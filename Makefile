@@ -1,9 +1,9 @@
-# Top-level build: libmxshim.so, libsedumi_b200.so (sm_100a CUDA) and the MEX stubs.
-# `make oracle` additionally builds the reference MEX targets into oracle/_ref (needs
-# /root/reference; test infrastructure only).
+# Top-level build: libmxshim.so, libsedumi_b200.so (sm_90a CUDA, H100) and the MEX stubs.
+# `make oracle` additionally builds the reference MEX targets into oracle/_ref (needs a
+# checkout of the reference, REF=<dir>; test infrastructure only).
 NVCC     ?= /usr/local/cuda/bin/nvcc
 CXX      ?= g++
-ARCH     := -gencode arch=compute_100a,code=sm_100a
+ARCH     := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS  := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Iinclude -Isedumi_b200/csrc --fmad=true $(if $(FUSED_PROF),-DSB200_FUSED_PROF)
 CSRC     := $(wildcard sedumi_b200/csrc/*.cu)
 COBJ     := $(CSRC:.cu=.o)

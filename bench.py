@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- IPM iterations/s over SeDuMi's normal-equations hot path on B200.
+"""bench.py -- IPM iterations/s over SeDuMi's normal-equations hot path on an H100.
 
-Contract: `python bench.py --gpus N --steps K --warmup W [--impl reference]` prints ONE JSON line.
+Contract: `python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]` prints ONE JSON line.
 A "step" is one pass of the per-iteration recipe (SURVEY 8d; sedumi.m:442-466, wrapPcg.m:56-59,
 updtransfo.m:99-108) over the frozen state of the workload:
 
@@ -19,8 +19,11 @@ order 200 and m=5000 constraints (arrow-shaped ADA: 64 elimination-tree subtrees
 `e2e`   = the same recipe with HOST buffers: at N=1 through the reference-facing MEX plugins (every call copies
           in and out), at N>1 through the device API with pinned host buffers copied in/out every step;
 `parity` = the SURVEY 8d gates evaluated in this run, before the timed region, against one reference iteration on
-          the same inputs (oracle/gates.py); that reference iteration is also the `cpu_baseline` sample;
+          the same inputs (oracle/gates.py; needs the reference build oracle/_ref, otherwise reported as not run);
+          that reference iteration is also the `cpu_baseline` sample;
 `secondary` = control07 / nb / arch0 / maxcut4000 (the other BASELINE configs) on one GPU, each with its own gates.
+--dump-outputs DIR writes what the last timed step of the headline workload computed (rank 0) as DIR/<name>.npy, float64;
+an output of more than DUMP_MAX elements is a fixed, seeded sample of that many of its entries.
 """
 import argparse
 import json
@@ -92,7 +95,7 @@ def load_workload(name):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region (read-only queries, 50 ms apart)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -291,7 +294,22 @@ def run_reference(W, steps, warmup, sample_blocks=0):
 
 
 # ----------------------------------------------------------------------------- device-resident run
-def device_run(W, args, rank, world, local_rank, sharded, dist, steps, warmup, want_parity=True, flush_mb=256):
+DUMP_MAX = 1 << 19        # elements per dumped array (4 MB as float64): the 13 device outputs stay below 64 MB in all
+
+
+def dump_outputs(hp, S, outdir):
+    """What the device path hands its caller after an iteration (oracle/gates.py device_outputs), one .npy each."""
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
+    import gates
+    os.makedirs(outdir, exist_ok=True)
+    for name, a in gates.device_outputs(hp, S, int(S.L["L"].nnz)).items():
+        a = np.asarray(a, dtype=np.float64).ravel()
+        if a.size > DUMP_MAX:
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX, replace=False))]
+        np.save(os.path.join(outdir, name + ".npy"), a)
+
+
+def device_run(W, args, rank, world, local_rank, sharded, dist, steps, warmup, want_parity=True, flush_mb=256, dump=None):
     import torch
     from sedumi_b200 import device as sbdev
     S, d = W.S, W.d
@@ -345,8 +363,9 @@ def device_run(W, args, rank, world, local_rank, sharded, dist, steps, warmup, w
             hp.iteration(NSOLVE, NPSD, sharded)
         # ---- parity gates (untimed): the state the device holds after one iteration vs one reference iteration
         out.parity = None
-        if want_parity and rank == 0:
-            sys.path.insert(0, os.path.join(ROOT, "oracle"))
+        sys.path.insert(0, os.path.join(ROOT, "oracle"))
+        import replay
+        if want_parity and rank == 0 and replay.available():
             import gates
             if sharded and info is not None:
                 import ctypes as C
@@ -378,6 +397,8 @@ def device_run(W, args, rank, world, local_rank, sharded, dist, steps, warmup, w
         if not args.no_graph:
             launches = hp.launches_per_iteration * steps      # kernels inside the replayed graphs
         out.launches = int(launches)
+        if dump and rank == 0:                        # after the launch count: the dump launches kernels of its own
+            dump_outputs(hp, S, dump)
         ms = sum(a.elapsed_time(b) for a, b in ev)
         # also a back-to-back (no flush) figure for context
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -418,21 +439,16 @@ def device_run(W, args, rank, world, local_rank, sharded, dist, steps, warmup, w
             peaks = measured_peaks()
             if w["bound"] == "hbm":
                 achieved = w["work"] / (per_iter_ms * 1e-3) / 1e9
-                peak = peaks.get("hbm_gbs", 6650.0)
-                src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
+                peak = peaks.get("hbm_gbs", 3350.0)
+                src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s"
             else:
                 achieved = w["work"] / (per_iter_ms * 1e-3) / 1e12
                 with torch.cuda.stream(torch.cuda.default_stream()):
                     peak = f64_gemm_peak(torch, dev)
                 src = ("FP64 (bound=tensor means the FP64 DMMA/FMA pipes): measured in-run, torch.matmul f64 4096^3 best of 5 "
                        "-- MEASURED_PEAKS.json has no FP64 entry")
-            traffic = None
-            try:        # DRAM bytes per iteration of that kernel from the committed ncu --set full capture
-                traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic_r02.json"))).get(W.name, {}).get(nm)
-            except (OSError, ValueError):
-                pass
             out.roof = {"kernel": nm, "bound": w["bound"], "achieved": achieved, "peak": peak, "unit": w["unit"],
-                        "frac": achieved / peak, "traffic": traffic, "peak_source": src, "work_model": w["what"],
+                        "frac": achieved / peak, "peak_source": src, "work_model": w["what"],
                         "algorithmic_bytes": w.get("bytes"),
                         "launches_per_step": cnt / nprof, "ms_per_step_in_kernel": per_iter_ms,
                         "share_of_step": tms / tot_ms,
@@ -581,7 +597,7 @@ def secondary_entry(name, args, local_rank):
     t0 = time.perf_counter()
     W = load_workload(name)
     big = name.startswith("maxcut4") or name.startswith("dense")
-    steps = 5 if big else 40
+    steps = args.steps
     out = device_run(W, args, 0, 1, local_rank, False, None, steps, 3, want_parity=not (big and args.quick_secondary))
     e = {"workload": DESCR[name][0], "value": steps / (out.ms_max * 1e-3), "unit": "iterations/s", "ms_per_step": out.ms_max / steps,
          "steps": steps, "gpu_launches_per_step": out.launches // steps,
@@ -594,9 +610,10 @@ def secondary_entry(name, args, local_rank):
         e["cpu_baseline"] = {"value": 1.0 / p["ref_seconds"], "unit": "iterations/s", "cores": 1, "kind": "reference",
                              "sample": "the one reference iteration of the parity gate"}
     else:
-        e["parity"] = "not run in the bench (see tests/test_fullsize_gpu.py)"
+        e["parity"] = ("not run by default (--full-secondary runs it; tests/test_fullsize_gpu.py checks it)" if big and args.quick_secondary else
+                       "not run: the reference build (oracle/_ref) is not present")
     if not big and not args.no_e2e:
-        e2 = run_e2e_mex(W, 10)
+        e2 = run_e2e_mex(W, args.steps)
         e["e2e"] = {k: e2[k] for k in ("value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step", "steps")}
     e["seconds_spent"] = round(time.perf_counter() - t0, 1)
     del out
@@ -609,6 +626,7 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     ap.add_argument("--workload", default=HEADLINE)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
@@ -671,7 +689,7 @@ def main():
             return bytes(t.cpu().tolist())
         sbdev.comm_init(rank, world, local_rank, bcast)
     out = device_run(W, args, rank, world, local_rank, sharded, dist if world > 1 else None, args.steps, args.warmup,
-                     want_parity=not args.no_parity)
+                     want_parity=not args.no_parity, dump=args.dump_outputs)
     config["parallelism"] = out.parallelism if sharded else (f"replicas x{world} (no data-path collective)" if world > 1 else "1 GPU")
     value = (1 if sharded else world) * args.steps / (out.ms_max * 1e-3)
     line = {"metric": METRIC, "value": value, "unit": "iterations/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -686,13 +704,12 @@ def main():
     if not args.no_e2e:
         if world > 1:
             dist.barrier()
-        nsteps_e2e = max(20, min(40, args.steps))
         if world == 1:
-            e2e = run_e2e_mex(W, nsteps_e2e if W.S.m < 2000 else 20)
+            e2e = run_e2e_mex(W, args.steps)
             e2e["route"] = "MEX plugins (reference-facing boundary), host buffers"
         else:
             local_x = out.hp.psd_x.cpu().numpy()[:out.hp.lenud]
-            e2e = e2e_device_api(W, out.hp, sharded, nsteps_e2e, world, dist, local_x)
+            e2e = e2e_device_api(W, out.hp, sharded, args.steps, world, dist, local_x)
             e2e["route"] = "device API with pinned host buffers (the MEX boundary is single-process / single-GPU)"
             if not sharded:
                 e2e["value"] *= world
@@ -713,6 +730,8 @@ def main():
                                         "sample": "1 full iteration of the same recipe on the same inputs (the one the parity gates compare against): "
                                                   f"reference mexFunctions (oracle/_ref, gcc -O2, single-threaded like the reference) + numpy psdscale, "
                                                   f"{p['ref_seconds']:.1f}s; harness marshalling excluded"}
+        elif not args.no_parity:
+            line["parity"] = "not run: the reference build (oracle/_ref) is not present"
         if not args.no_secondary and world == 1 and name == HEADLINE:
             sec = []
             for nm in [s for s in args.secondary.split(",") if s]:
@@ -728,7 +747,7 @@ def main():
         sys.stdout.flush()
         sys.stderr.flush()
         # The communicators (torch's and the library's) are torn down by process exit: destroying an NCCL communicator
-        # whose collectives live in instantiated CUDA graphs blocked for minutes on the B200 box (round-2 N=2 run).
+        # whose collectives live in instantiated CUDA graphs can block for minutes.
         os._exit(0)
 
 

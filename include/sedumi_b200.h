@@ -1,4 +1,4 @@
-/* sedumi_b200.h -- C-ABI of libsedumi_b200.so: the B200 (sm_100a) implementation of
+/* sedumi_b200.h -- C-ABI of libsedumi_b200.so: the H100 (sm_90a) implementation of
  * SeDuMi's per-iteration normal-equations hot path.
  *
  * Boundary contract.  The reference's FFI for this path is the MEX plugin interface:

@@ -3,7 +3,7 @@
  * points; reference call sites e.g. blkchol.c:239-440, getada3.c:370-569).
  *
  * Purpose: (1) lets the reference C sources compile unmodified into oracle/_ref/
- * for parity testing; (2) lets the B200 MEX stubs in sedumi_b200/mex/ be built and
+ * for parity testing; (2) lets the CUDA MEX stubs in sedumi_b200/mex/ be built and
  * driven from Python (ctypes) on a box that has neither MATLAB nor Octave.  On a
  * user's machine the same stubs compile against the real mex.h instead.
  *

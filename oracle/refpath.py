@@ -19,15 +19,16 @@ for _p in (_ROOT, _HERE):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
+import replay  # noqa: E402
 import restate  # noqa: E402
 from sedumi_b200.host import setup as hsetup  # noqa: E402
-from sedumi_b200.mx import MexDir  # noqa: E402
 
 CHOL_PARS = {"canceltol": 1e-12, "maxu": 5e5, "abstol": 1e-20}      # checkpars.m:150-170
 
 
-def ref_dir(debug=False) -> MexDir:
-    return MexDir(os.path.join(_HERE, "_ref", "dbg") if debug else os.path.join(_HERE, "_ref"))
+def ref_dir(debug=False) -> replay.OracleDir:
+    """The reference targets, answered from tests/golden/oracle where a record exists (oracle/replay.py)."""
+    return replay.OracleDir(debug)
 
 
 class RefHotPath:

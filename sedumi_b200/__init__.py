@@ -1,2 +1,2 @@
-"""sedumi_b200 -- B200-native normal-equations hot path behind SeDuMi's MEX boundary."""
+"""sedumi_b200 -- H100-native normal-equations hot path behind SeDuMi's MEX boundary."""
 __version__ = "0.1.0"

@@ -919,7 +919,7 @@ static int ada_build(sb200_ada_plan *pl, sb_idx N, sb_idx m, const sb_idx *Ajc, 
       // dense products first, then the entry-wise pairs; inside a class BLOCK BY BLOCK (then dearest first): the resident
       // CTAs then share two or three blocks' D_k and partner entries in L2.  Handing the pairs out by cost alone
       // interleaved all blocks (pair numbering follows the constraints): 91 MB of partner entries + 47 MB of T slots
-      // + 20 MB of D for the 64 x 200 problem do not fit the 126 MB L2, and ncu showed 2.0 GB of DRAM traffic per launch.
+      // + 20 MB of D for the 64 x 200 problem, far more than the 50 MB L2 of an H100.
       std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
         const int ca = pl->pairs[a].mode != 0, cb = pl->pairs[b].mode != 0;
         if (ca != cb) return ca < cb;
@@ -929,7 +929,7 @@ static int ada_build(sb200_ada_plan *pl, sb_idx N, sb_idx m, const sb_idx *Ajc, 
       if (need_pq.empty()) need_pq.push_back(0);
       SB_TRY(pl->d_fneed.upload(need_pq)); SB_TRY(pl->d_forder.upload(order));
       // ---- strips: (pair, column strip) work items for blocks that leave no room for a second resident CTA
-      if (!pl->fused_small && getenv("SB200_STRIP_ADA3")) {         // opt-in: measured slower than the whole-pair kernel (DESIGN.md)
+      if (!pl->fused_small && getenv("SB200_STRIP_ADA3")) {         // opt-in, parity-tested alternative to the whole-pair kernel (DESIGN.md)
         bool sok = true;
         std::vector<int> bgb(nblk + 1, 0);
         std::vector<StripGroup> groups;

@@ -9,8 +9,8 @@
 //      packed lower triangle of W;
 //   3. every constraint i of block k that precedes j in the ordering takes <A_ik, W> from shared memory
 //      (dots_partners, the same code the unfused kernel uses), writes ADA(i,j) / per-pair partial sums and absd.
-// The unfused path materialised W (n^2 doubles per pair) in HBM between a GEMM launch and a dots launch: 7x the
-// algorithmic traffic of getada3 (profiles/traffic_r01.json).  Reference: getada3.c:305-351, spscale.c:249-305.
+// The unfused path materialised W (n^2 doubles per pair) in HBM between a GEMM launch and a dots launch: several
+// times the algorithmic traffic of getada3.  Reference: getada3.c:305-351, spscale.c:249-305.
 #pragma once
 
 namespace sb {
@@ -19,7 +19,7 @@ static const int FUSED_MAX_N = 208;                 // 7 x 7 supertiles -> 28 wa
 static const int FKC = 8;                            // k-slab depth (two DMMA k-steps)
 static const int FUSED_GEMM_WARPS = 16;              // warps that hold a 32x32 accumulator tile in one round
 static const int FTK = 8, FTST = 2;                  // TMA ring: k-depth of a slab, stages (FTK * FTST == 2 * FKC: same shared memory;
-                                                     // 4 x 4 measured 17 % slower: twice the barrier hand-overs per DMMA)
+                                                     // 4 x 4 is slower: twice the barrier hand-overs per DMMA)
 
 struct FusedArgs {
   const AdaPair *pairs; int npairs;

@@ -2,8 +2,7 @@
 //
 // ada_fused.cuh keeps the whole packed lower triangle of W_jk in shared memory (160 KB at n = 200): one CTA per SM, and
 // its phases -- T = sym(A_jk) D (L2 latency), W = D T (FP64 tensor pipe), <A_ik, W> (L2 latency + shared memory) -- run
-// one after the other with nothing to overlap them (ncu r02: DMMA pipe 28-38 % busy over the kernel although the
-// product phase itself runs it at ~80 %).  Here the unit of work is a (pair, column strip) instead of a pair:
+// one after the other with nothing to overlap them (the DMMA pipe idles outside the product phase).  Here the unit of work is a (pair, column strip) instead of a pair:
 //   * the lower triangle is cut into strips of whole supertile columns (<= STRIP_WCAP entries, <= 8 supertiles: one
 //     round of 8 warps); a strip is a CONTIGUOUS range of the packed index, so W_strip is a plain sub-array;
 //   * only the strip's columns of T are built (the strips of a pair partition T: no work is duplicated) and only rows

@@ -1,4 +1,4 @@
-// chol.cu -- supernodal sparse LDL' on B200: numeric factorisation with SeDuMi's pivot
+// chol.cu -- supernodal sparse LDL' on H100: numeric factorisation with SeDuMi's pivot
 // safeguards, and the forward/backward block solves.
 //
 // Reference semantics reproduced (not its code structure):

@@ -107,9 +107,9 @@ dense_ldl_kernel(int m, double *W, double *Lo, double *d, const double *lb, cons
       __syncthreads();
       int k_resume = 0, resolved_k = -1;
       // All 8 warps cooperate on each pivot step: the lower triangle below/right of the pivot is at most 31*32/2
-      // elements, one per thread.  (Round 2 tried one warp holding the block in registers with the pivot column moved
-      // by shuffles -- ldl_block.cuh, used by the supernodal kernel: as part of THIS kernel it measured 1.8x slower,
-      // the single warp is issue-bound on 31 shuffle/multiply/FMA triples per pivot.)
+      // elements, one per thread.  (One warp holding the block in registers with the pivot column moved by shuffles --
+      // ldl_block.cuh, used by the supernodal kernel -- is slower as part of THIS kernel: the single warp is
+      // issue-bound on 31 shuffle/multiply/FMA triples per pivot.)
       while (true) {
         {
         int k = k_resume;
@@ -134,7 +134,7 @@ dense_ldl_kernel(int m, double *W, double *Lo, double *d, const double *lb, cons
           }
           __syncthreads();
           // (scaling the column one step later, in the shadow of the next update, saves a barrier but
-          // measured 17 % slower: the extra loop-carried state lengthens the dependent chain)
+          // is slower: the extra loop-carried state lengthens the dependent chain)
           if (tid > k && tid < w) A[tid][k] *= rinv;
           if (tid == 0) { dloc[k] = xkk; A[k][k] = 1.0; }
           __syncthreads();
@@ -431,7 +431,7 @@ static const int SOLVE_CLUSTER = 8;
 __device__ __forceinline__ void fence_cluster() { asm volatile("fence.acq_rel.cluster;\n" ::: "memory"); }
 // Hand-over of a solved block row inside the cluster: the producer writes y_b into every CTA's shared memory with
 // st.async, which also counts the bytes on an mbarrier of the RECEIVING CTA; consumers sleep on their local mbarrier
-// (try_wait is a hardware wait, not a poll).  One DSMEM hop (~215 cycles) + wake-up (~60) per dependent block row,
+// (try_wait is a hardware wait, not a poll).  One DSMEM hop + wake-up per dependent block row,
 // instead of store + cluster fence + flag + polling.
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) {

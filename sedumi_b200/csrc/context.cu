@@ -116,7 +116,7 @@ Hash128 hash128(const void *data, size_t bytes, Hash128 seed) {
 // D2H: the DMAs of one set are enqueued, the previous set is drained to the destination by the host threads; the call
 // returns when the destination is complete (again what the pageable call does).
 namespace {
-struct CopyPool {            // plain mutex / condition-variable fork-join: jobs are 2 MB memcpy's, ~100 us each
+struct CopyPool {            // plain mutex / condition-variable fork-join: jobs are 2 MB memcpy's
   std::vector<std::thread> th;
   std::mutex mu;
   std::condition_variable cv_job, cv_done;
@@ -394,7 +394,7 @@ int sb200_init(int device) {
   sb::Context &c = sb::ctx();
   if (c.inited && c.device == device) return 0;
   int n = sb200_device_count();
-  if (n <= 0) { sb::set_error("sb200_init: no CUDA device visible (the B200 path has no CPU fallback)"); return 1; }
+  if (n <= 0) { sb::set_error("sb200_init: no CUDA device visible (the GPU path has no CPU fallback)"); return 1; }
   if (device < 0 || device >= n) { sb::set_error("sb200_init: device %d out of range (%d visible)", device, n); return 1; }
   SB_CUDA(cudaSetDevice(device));
   if (c.stream) { cudaStreamDestroy(c.stream); c.stream = nullptr; }

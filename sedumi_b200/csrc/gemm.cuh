@@ -9,7 +9,7 @@
 // (per-PSD-block / per-constraint problems of different sizes), so the grid scales with
 // the total work, not with the number of problems.
 //
-// FP64 on sm_100a has no tcgen05 kind; the tensor path for doubles is the legacy
+// FP64 on sm_90a has no wgmma kind; the tensor path for doubles is the legacy
 // mma.sync m8n8k4 DMMA, used by the 64x64 tile kernel below (each warp owns a 32x32
 // sub-tile = 4x4 DMMA fragments).  Operands are staged through shared memory.
 #pragma once
@@ -136,11 +136,10 @@ __device__ __forceinline__ void gemm_warp_mma(double (&acc)[4][4][2], const doub
 // tile (16 DMMAs per 8 shared-memory fragment loads) and, inside every k-slab, the k4-steps of its
 // k-group (w>>2); the two partial tiles are added through shared memory at the end.  Splitting k inside
 // the CTA keeps 8 warps busy per tile: the per-block products here often have fewer tiles than the GPU
-// has SMs (ncu, n=1000: 256 tiles, 9 % warp occupancy with 4 warps per tile).
+// has SMs (n = 1000: 256 tiles, against 132 SMs; 4 warps per tile leave most warp slots empty).
 // KG = 1 (128 threads, no split) is used when a launch has tiles to spare: more CTAs per SM.
 // GST-stage cp.async pipeline: slabs s+1..s+GST-1 are in flight while the DMMAs of slab s run (with two
-// stages the copy of the next slab was issued one slab-time (~250 cycles at full DMMA rate) before it was
-// needed, less than the L2 latency).
+// stages the copy of the next slab is issued one slab-time before it is needed, less than the L2 latency).
 template <int KG, int GKT>
 static __global__ void __launch_bounds__(128 * KG)
 gemm_nt_kernel(const GemmDesc *descs, const GemmTile *tiles, const double *baseA, const double *baseB,

@@ -54,7 +54,7 @@ __device__ void d_givensrotuj(double *z, const double *g, int n) {
 struct UrotBlk { int n; long long uoff; int poff; long long goff; };   // goff: in doubles, worst-case layout
 
 // ---- speculative "nothing to rotate" pre-pass for large blocks.  The column-pivoting loop below is n dependent steps
-// (17 ms at n = 4000) even when no pivot is ever exchanged, which is the common case.  If no exchange happens, every
+// even when no pivot is ever exchanged, which is the common case.  If no exchange happens, every
 // decision of the loop depends on the ORIGINAL factor only: d0(i) = sum_{t<=i} u(t,i)^2 (computed once, at k = 0) and
 // rowmax(k) = max_{j>k} u(k,j)^2.  Both are computed here in parallel -- d0 with the reference's summation order, so
 // the comparisons are the reference's bit for bit -- and the loop is skipped when every test comes out "keep".

@@ -56,7 +56,7 @@ static __device__ __noinline__ int warp_factor_block(double (*A)[LDLB + 1], cons
 // The same for an 8 x 8 diagonal block, fully unrolled and branch-free (lanes 0..7 hold the rows): 28 shuffle / FMA
 // steps.  Used by the supernodal panel kernel, whose blocked pass advances 8 columns at a time -- the 32-wide version
 // above costs ~1 600 instructions per pivot on a single warp (sliding-window moves, predicated selects and a
-// WARPSYNC/ENDCOLLECTIVE pair around every shuffle), 30 us per block.
+// WARPSYNC/ENDCOLLECTIVE pair around every shuffle).
 static const int LDLS = 8;
 static __device__ __forceinline__ int warp_factor_block8(double (*A)[LDLS + 1], const double *s_lb, double *dloc, int *skipped, int *flag,
                                                          double *sval, int p0, int w, int m, double ub) {

@@ -12,7 +12,7 @@
 namespace sb {
 
 // a group of G lanes per (block, column): dot over the block's rows.  G follows the average cone length so that short
-// cones do not pay a 5-step shuffle reduction for two elements per lane (cones of 64: 67 % -> see profiles/).
+// cones do not pay a 5-step shuffle reduction for two elements per lane.
 template <int G>
 __global__ void ddot_dense_kernel(int nblk, const long long *bs, const double *d, const double *X, long long ldx,
                                   long long ncol, double *y) {

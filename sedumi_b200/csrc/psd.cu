@@ -284,7 +284,7 @@ wy_tinv_big_kernel(const int *pblk, const int *pidx, const int *ns, const long l
 // and streams each panel V_p (rows c0..n-1, 32 reflectors) twice through a double-buffered cp.async
 // ring: once for Y = R V_p, once for R -= (Y T_p') V_p'.  Compared with one warp per column applying the
 // reflectors one by one, the 8 columns share every load of V (8x less L2 traffic, which bounded that
-// kernel: 2.7 ms per call at n=1000) and the dot/axpy pairs become two small matrix products.
+// kernel) and the dot/axpy pairs become two small matrix products.
 static const int WY_RW = 8, WY_CH = 128;
 __global__ void __launch_bounds__(256)
 wy_rows_kernel(const int *grp_blk, const int *grp_j0, const int *ns, const long long *offs, const long long *toff,
@@ -764,8 +764,8 @@ static int psd_build(sb200_psd_plan *pl, sb_idx nblk, const sb_idx *n) {
   {
     const int nld = (pl->maxn + 1) & ~1;
     pl->wy_rows_smem = sizeof(double) * ((size_t)WY_RW * nld + 2 * WY_CH * (WYB + 1) + 2 * WY_RW * WYB + WYB * (WYB + 1));
-    // small blocks: the one-warp-per-column kernel is a single short launch (47 us at n=70 against 65 us
-    // for T factors + row kernel)
+    // small blocks: the one-warp-per-column kernel is a single short launch (the row kernel needs the T factors
+    // first: two launches)
     pl->wy_rows = pl->maxn > 96 && pl->wy_rows_smem <= 220 * 1024;
     if (const char *e = getenv("SB200_WY_GEMM_MIN_N")) if (pl->maxn >= atoi(e)) pl->wy_rows = false;     // tests: force the GEMM path
     pl->wy = pl->maxn > 96 && !pl->wy_rows;
@@ -1057,8 +1057,8 @@ static int build_q(sb200_psd_plan *pl, const double *frms_dev, bool need_transpo
   }
   if (pl->wy) {
     // R = Q' accumulated right to left, panel by panel:  R <- R (I - V_p T_p V_p')' = R - (R V_p) T_p' V_p'
-    // with panels of 128 reflectors, so that every product of the loop has N or K = 128 (with 32-wide panels the
-    // rank-32 updates were 75 of the 150 ms the n = 4000 block spent in the GEMM engine)
+    // with panels of 128 reflectors, so that every product of the loop has N or K = 128 (32-wide panels make the
+    // rank-32 updates the bulk of the GEMM-engine time of a large block)
     transpose_scale_kernel<<<dim3(std::min(1024, tp * tp), pl->nblk), dim3(32, 8), 0, st>>>(pl->d_n.p, pl->d_off.p, pl->d_poff.p, frms_dev, nullptr, pl->d_Xp.p);   // F'
     SB_LAUNCH_CHECK_N("transpose_scale_kernel");
     gemm_nt_launch(pl->wy_gn, ctx().sm_count, st, pl->d_wy_desc.p, pl->d_wy_tiles.p + pl->wy_gt, pl->d_Xp.p, pl->d_Xp.p, pl->d_wy_G.p, nullptr);

@@ -14,7 +14,7 @@ namespace sb {
 struct Context {
   bool inited = false;
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;                      // H100 SXM; replaced by the device's count in ensure_init()
   cudaStream_t stream = nullptr;
   int64_t launches = 0;
   int64_t h2d_bytes = 0, d2h_bytes = 0;   // bytes moved over PCIe by this library (every cudaMemcpyAsync, counted below)

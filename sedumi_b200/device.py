@@ -37,7 +37,7 @@ def lib() -> C.CDLL:
     global _lib
     if _lib is None:
         if not os.path.exists(_LIB_PATH):
-            raise ImportError(f"{_LIB_PATH} missing: run __graft_entry__.build() (nvcc, sm_100a) first")
+            raise ImportError(f"{_LIB_PATH} missing: run __graft_entry__.build() (nvcc, sm_90a) first")
         L = C.CDLL(_LIB_PATH)
         L.sb200_last_error.restype = C.c_char_p
         L.sb200_kernel_launches.restype = I64

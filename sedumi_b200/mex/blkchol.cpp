@@ -1,4 +1,4 @@
-// [LL,Ld,Lskip,Ladd] = blkchol(L,X[,pars[,absd]])  -- B200 plugin, same contract as the
+// [LL,Ld,Lskip,Ladd] = blkchol(L,X[,pars[,absd]])  -- CUDA plugin, same contract as the
 // reference MEX (blkchol.c:58-69 signature, :239-440 mexFunction).
 #include "mex_common.h"
 
@@ -27,7 +27,7 @@ void mexFunction(int nlhs, mxArray *plhs[], int nrhs, const mxArray *prhs[]) {
     if ((f = mxGetField(PARS, 0, "maxu")) != NULL) pars.maxu = mxGetScalar(f);
     if ((f = mxGetField(PARS, 0, "abstol")) != NULL) { pars.abstol = mxGetScalar(f); if (pars.abstol < 0.0) pars.abstol = 0.0; }
     if ((f = mxGetField(PARS, 0, "delay")) != NULL && mxGetScalar(f) != 0.0)
-      mexErrMsgTxt("blkchol: pars.delay is not supported by the B200 plugin (sedumi.m never sets it).");
+      mexErrMsgTxt("blkchol: pars.delay is not supported by the CUDA plugin (sedumi.m never sets it).");
     if (nrhs >= 4) {
       MEX_REQUIRE(numel(prhs[3]) == m, "absd size mismatch");
       absd = mxGetPr(prhs[3]);

@@ -19,7 +19,7 @@ void mexFunction(int nlhs, mxArray *plhs[], int nrhs, const mxArray *prhs[]) {
   const mxArray *B = prhs[1];
   MEX_REQUIRE(mxGetM(B) == m, "Size mismatch b.");
   if (mxIsSparse(B))
-    mexErrMsgTxt("bwblkslv: sparse right-hand sides are not supported by the B200 plugin "
+    mexErrMsgTxt("bwblkslv: sparse right-hand sides are not supported by the CUDA plugin "
                  "(SeDuMi only calls bwblkslv with full b, sparbwslv.m:48).");
   mwSize n = mxGetN(B);
   plhs[0] = mxCreateDoubleMatrix(m, n, mxREAL);

@@ -6,7 +6,7 @@ void mexFunction(int nlhs, mxArray *plhs[], int nrhs, const mxArray *prhs[]) {
   MEX_REQUIRE(nlhs <= 2, "psdfactor generates 2 output arguments.");
   ConeK K;
   read_cone(prhs[1], K);
-  MEX_REQUIRE(K.rsdpN == K.sdpN, "psdfactor: Hermitian PSD blocks are not handled by the B200 plugin");
+  MEX_REQUIRE(K.rsdpN == K.sdpN, "psdfactor: Hermitian PSD blocks are not handled by the CUDA plugin");
   const sb_idx N = K.rDim;
   MEX_REQUIRE((sb_idx)numel(prhs[0]) >= N, "x size mismatch");
   plhs[0] = mxCreateDoubleMatrix((mwSize)N, 1, mxREAL);

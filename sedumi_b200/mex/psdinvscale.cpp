@@ -7,7 +7,7 @@ void mexFunction(int nlhs, mxArray *plhs[], int nrhs, const mxArray *prhs[]) {
   ConeK K;
   read_cone(prhs[2], K);
   if (K.sdpN == 0) { plhs[0] = mxCreateDoubleMatrix(0, 0, mxREAL); return; }
-  MEX_REQUIRE(K.rsdpN == K.sdpN, "psdinvscale: Hermitian PSD blocks are not handled by the B200 plugin");
+  MEX_REQUIRE(K.rsdpN == K.sdpN, "psdinvscale: Hermitian PSD blocks are not handled by the CUDA plugin");
   const sb_idx N = K.rDim;
   MEX_REQUIRE((sb_idx)numel(prhs[0]) >= N, "ud size mismatch");
   MEX_REQUIRE((sb_idx)numel(prhs[1]) >= N && !mxIsSparse(prhs[1]), "x size mismatch");

@@ -6,7 +6,7 @@ void mexFunction(int nlhs, mxArray *plhs[], int nrhs, const mxArray *prhs[]) {
   MEX_REQUIRE(nlhs <= 2, "qrK produces less output arguments");
   ConeK K;
   read_cone(prhs[1], K);
-  MEX_REQUIRE(K.rsdpN == K.sdpN, "qrK: Hermitian PSD blocks are not handled by the B200 plugin");
+  MEX_REQUIRE(K.rsdpN == K.sdpN, "qrK: Hermitian PSD blocks are not handled by the CUDA plugin");
   const sb_idx sdpdim = K.rDim + K.hDim;
   MEX_REQUIRE((sb_idx)numel(prhs[0]) == sdpdim, "size mismatch x");
   mxArray *Q = mxCreateDoubleMatrix((mwSize)(sdpdim + K.hLen), 1, mxREAL), *R = mxCreateDoubleMatrix((mwSize)sdpdim, 1, mxREAL);

@@ -3,7 +3,7 @@
 This is the host side of the MEX boundary when no MATLAB/Octave interpreter is
 present: Python plays the interpreter's role and calls ``mexFunction`` in a plugin
 ``.so`` exactly as MATLAB would (SURVEY.md section 8b; reference plugins e.g.
-blkchol.c:239, getada3.c:370).  The same marshalling drives both the B200 plugins in
+blkchol.c:239, getada3.c:370).  The same marshalling drives both the CUDA plugins in
 ``sedumi_b200/mex/`` and (in tests / the CPU baseline only) the reference plugins in
 ``oracle/_ref/``.
 

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _has_gpu():
@@ -19,6 +19,15 @@ def _has_gpu():
         return lib.sb200_device_count() > 0
     except OSError:
         return False
+
+
+@pytest.fixture(autouse=True)
+def _reference_answers(request):
+    """After each test: write its recorded reference answers, or check that it asked for all of them."""
+    yield
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
+    import replay
+    replay.finish(request.node.nodeid)
 
 
 def pytest_collection_modifyitems(config, items):

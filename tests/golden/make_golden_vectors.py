@@ -1,9 +1,10 @@
 """Generate golden input/output vectors for the hot path from the reference itself.
 
-Runs the UNMODIFIED reference MEX targets (oracle/_ref, built from /root/reference by
-oracle/Makefile) on small seeded inputs and stores inputs + outputs as .npz.  The reference holds
-no per-kernel vectors of its own (SURVEY.md section 8c), so these files -- produced by the
-reference's code on this container -- are the known-answer tests that travel to the GPU box.
+Runs the UNMODIFIED reference MEX targets (oracle/_ref, built by `make -C oracle REF=<checkout>`)
+on small seeded inputs and stores inputs + outputs as .npz.  The reference holds no per-kernel
+vectors of its own (SURVEY.md section 8c), so these files -- produced by the reference's own code --
+are the known-answer tests of the suite.  (The answers the GPU parity tests compare against are
+recorded separately: SEDUMI_ORACLE=record python -m pytest tests, see oracle/replay.py.)
 
     python tests/golden/make_golden_vectors.py
 """

@@ -1,7 +1,7 @@
 """Convert the reference's example problems into portable .npz fixtures.
 
-Run in the build container (needs /root/reference):  python tests/golden/make_problem_fixtures.py
-The GPU box has no /root/reference, so bench.py / -m gpu tests read these files instead
+Needs a checkout of the reference:  python tests/golden/make_problem_fixtures.py <reference checkout>
+bench.py and the tests read these files, so they run without the reference
 (examples/README.md in the reference documents the provenance of the .mat files).
 Only the raw problem data (At, b, c, K) is stored -- no reference code.
 """
@@ -12,7 +12,7 @@ import numpy as np
 import scipy.io as sio
 import scipy.sparse as sp
 
-REF = "/root/reference/examples"
+REF = os.path.join(sys.argv[1], "examples")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "problems")
 NAMES = ["arch0", "control07", "nb", "trto3"]
 

@@ -1,10 +1,12 @@
 """Shared test helpers: the two plugin directories and small problem builders.
 
-`ref`  = the UNMODIFIED reference MEX targets compiled into oracle/_ref (the oracle),
-`dbg`  = the same with mxAssert active (validates what our host code marshals),
-`gpu`  = the B200 plugins (sedumi_b200/mex), which fail loudly without a CUDA device.
+`ref`  = the UNMODIFIED reference MEX targets compiled into oracle/_ref (the oracle), answered from the
+         records under tests/golden/oracle where one exists (oracle/replay.py),
+`dbg`  = the same with mxAssert active (validates what our host code marshals when called live),
+`gpu`  = the CUDA plugins (sedumi_b200/mex), which fail loudly without a CUDA device.
 """
 import os
+import sys
 
 import numpy as np
 import scipy.sparse as sp
@@ -12,14 +14,31 @@ import scipy.sparse as sp
 from sedumi_b200.mx import MexDir
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ref = MexDir(os.path.join(ROOT, "oracle", "_ref"))
-dbg = MexDir(os.path.join(ROOT, "oracle", "_ref", "dbg"))
+sys.path.insert(0, os.path.join(ROOT, "oracle"))
+import refpath  # noqa: E402
+import replay  # noqa: E402
+
+ref = refpath.ref_dir()
+dbg = refpath.ref_dir(debug=True)
 gpu = MexDir(os.path.join(ROOT, "sedumi_b200", "mex"))
 
 CHOL_PARS = {"canceltol": 1e-12, "maxu": 5e5, "abstol": 1e-20}      # checkpars.m:150-170
 
 
+def needs_reference(module, target):
+    """Skip unless the reference can answer: oracle/_ref built, or answers recorded for the test module."""
+    import pytest
+    return pytest.mark.skipif(not (ref.has(target) or replay.has_records(module)),
+                              reason="oracle/_ref not built and no recorded answers")
+
+
 def relerr(a, b):
+    """||a - b|| / ||b||; b may be a recorded reference output kept as a sketch (oracle/replay.py), then the
+    numerator is estimated from the sketch (exactly 0 when a holds the recorded bytes)."""
+    if isinstance(b, replay.Sketch):
+        a = np.asarray(a.todense() if sp.issparse(a) else a, dtype=float)
+        assert a.size == b.size, (a.shape, b.shape)
+        return b.error_norm(a if a.shape == b.shape else a.ravel()) / (b.norm if b.norm > 0 else 1.0)
     a = np.asarray(a.todense() if sp.issparse(a) else a, dtype=float)
     b = np.asarray(b.todense() if sp.issparse(b) else b, dtype=float)
     if a.shape != b.shape:                       # (N,1) against (N,): compare element by element, never broadcast
@@ -27,6 +46,13 @@ def relerr(a, b):
         a, b = a.ravel(), b.ravel()
     nb = np.linalg.norm(b)
     return np.linalg.norm(a - b) / (nb if nb > 0 else 1.0)
+
+
+def same(a, b):
+    """Bit equality of two arrays; b may be a recorded reference output kept as a sketch (compared by SHA-256)."""
+    if isinstance(b, replay.Sketch):
+        return b.matches(a)
+    return np.size(a) == np.size(b) and np.array_equal(np.ravel(a, order="F"), np.ravel(b, order="F"))
 
 
 def dense_L(m):
@@ -64,7 +90,7 @@ def full_pattern(X):
 
 
 def check_chol(L, X, pars, absd, tol=1e-10):
-    """Run oracle and B200 blkchol on the same inputs and compare all four outputs."""
+    """Run oracle and CUDA blkchol on the same inputs and compare all four outputs."""
     args = (L, X, pars) if absd is None else (L, X, pars, absd)
     LLr, dr, skr, adr = ref.blkchol(*args, nlhs=4)
     LLg, dg, skg, adg = gpu.blkchol(*args, nlhs=4)

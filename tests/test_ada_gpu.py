@@ -1,4 +1,4 @@
-"""Parity of the B200 invcholfac / getada1 / getada2 / getada3 / psdscale plugins against the
+"""Parity of the CUDA invcholfac / getada1 / getada2 / getada3 / psdscale plugins against the
 reference (oracle/_ref MEX for the C targets, oracle/restate.py for the M-only psdscale),
 through the same mexFunction boundary.  Gates: ADA, absd, udsqr <= 1e-10 relative."""
 import os

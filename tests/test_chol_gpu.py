@@ -1,4 +1,4 @@
-"""Parity of the B200 blkchol / fwblkslv / bwblkslv plugins against the reference MEX
+"""Parity of the CUDA blkchol / fwblkslv / bwblkslv plugins against the reference MEX
 (oracle/_ref), called through the same mexFunction boundary on the same inputs.
 Gates (SURVEY.md section 8d): L, d <= 1e-10 relative; identical skip/add index sets."""
 import numpy as np
@@ -87,9 +87,11 @@ def test_arrow_structure():
 
 @pytest.mark.parametrize("m,nrhs", [(1, 1), (50, 1), (300, 3), (666, 1)])
 def test_solves_dense(m, nrhs):
+    """Both solves on the same factor; it comes from the CUDA blkchol (checked against the reference above), so that
+    the reference's answers for this test stay small enough to store."""
     X = random_spd(m, seed=m + 17, cond=1e3)
     L = dense_L(m)
-    LL, d = ref.blkchol(L, full_pattern(X), CHOL_PARS, np.diag(X).copy(), nlhs=2)
+    LL, d = gpu.blkchol(L, full_pattern(X), CHOL_PARS, np.diag(X).copy(), nlhs=2)
     Lf = dict(L, L=LL)
     b = np.random.default_rng(m).standard_normal((m, nrhs))
     yr, yg = ref.fwblkslv(Lf, b), gpu.fwblkslv(Lf, b)

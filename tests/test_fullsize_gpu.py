@@ -53,7 +53,8 @@ def test_invcholfac_n1000_matches_numpy():
 
 # ---- oracle parity at BASELINE.json's full sizes: the device-resident pipeline against one reference iteration
 # (oracle/gates.py: ADA/absd/L/d 1e-10, identical skip/add sets, search direction 1e-8, PSD tail 1e-10 / bit-exact).
-# The reference needs about half a minute (blockdiag64) / a minute (maxcut4000) of one host core for it.
+# The reference needs minutes of one host core for it, so its iteration is recorded (oracle/replay.py: result;
+# large outputs as sketches, see tests/helpers.py relerr) and replayed.
 def _gated_iteration(name, nsolve=2, npsd=2, tail=True):
     import os
     import sys

@@ -3,10 +3,10 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
-from helpers import dbg, ref
+from helpers import dbg, needs_reference, ref
 from sedumi_b200.host import cones, problems, setup, symbolic
 
-needs_ref = pytest.mark.skipif(not ref.has("partitA"), reason="oracle/_ref not built")
+needs_ref = needs_reference("test_host", "partitA")
 
 
 def test_pretransfo_layout_control07():

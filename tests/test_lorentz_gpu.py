@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
-from helpers import gpu, ref, relerr
+from helpers import gpu, ref, relerr, same
 from sedumi_b200.host import cones, problems, setup
 
 pytestmark = pytest.mark.gpu
@@ -20,7 +20,7 @@ def test_quadadd_bit_exact():
     xhi[::11] = 0.0
     zr = ref.quadadd(xhi, xlo, y, nlhs=2)
     zg = gpu.quadadd(xhi, xlo, y, nlhs=2)
-    assert np.array_equal(zr[0], zg[0]) and np.array_equal(zr[1], zg[1])
+    assert same(zg[0], zr[0]) and same(zg[1], zr[1])
 
 
 def test_quadadd_empty():

@@ -15,7 +15,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import refpath  # noqa: E402
 import restate  # noqa: E402
 
-needs_ref = pytest.mark.skipif(not ref.has("blkchol"), reason="oracle/_ref not built (needs /root/reference)")
+needs_ref = pytest.mark.skipif(not ref.has("blkchol"), reason="oracle/_ref not built (needs a reference checkout)")
 
 
 @needs_ref

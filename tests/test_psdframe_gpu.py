@@ -13,11 +13,11 @@ def _K(s):
     return cones.finish_K({"l": 2.0, "q": np.array([3.0]), "s": np.array(s, dtype=float)})
 
 
-def _frames(K, seed):
+def _frames(K, seed, qr=ref):
     rng = np.random.default_rng(seed)
     blocks = [rng.standard_normal((int(n), int(n))) for n in K["s"]]
     x = np.concatenate([b.ravel(order="F") for b in blocks])
-    return ref.qrK(x, cones.K_for_mex(K))            # vfrm.s layout: reflectors + beta column
+    return qr.qrK(x, cones.K_for_mex(K))             # vfrm.s layout: reflectors + beta column
 
 
 @pytest.mark.parametrize("s", [(1,), (2,), (7,), (33, 5), (70, 35), (130,), (200, 40), (257,), (129, 2, 161)])
@@ -112,12 +112,14 @@ def test_urotorder_no_rotation_needed():
 def test_psdframeit_gemm_wy_path_wide_panels(monkeypatch):
     """Blocks beyond ~2300 accumulate Q through the tile-GEMM engine with 128-reflector panels (compact WY).  The
     path is forced at a size the reference handles quickly (the plan cache is keyed by the block sizes: 301 and 143
-    appear nowhere else in the suite)."""
+    appear nowhere else in the suite).  The frames come from the CUDA qrK (checked against the reference's in
+    tests/test_psdalg_gpu.py) and go to both sides, so that the reference's answers for this test stay small enough to
+    store."""
     monkeypatch.setenv("SB200_WY_GEMM_MIN_N", "100")
     s = (301, 143)
     K = _K(s)
     Km = cones.K_for_mex(K)
-    frms = _frames(K, 77)
+    frms = _frames(K, 77, qr=gpu)
     rng = np.random.default_rng(3)
     lab = rng.uniform(0.1, 3.0, int(sum(s)))
     assert relerr(gpu.psdframeit(lab, frms, Km), ref.psdframeit(lab, frms, Km)) <= 1e-10

@@ -1,6 +1,6 @@
 """world_size-2 gloo test of the multi-GPU sharding logic (host side): block partition, row shards,
 and the single all-reduce at the Schur-assembly boundary.  The per-rank compute is the oracle
-(reference getada chain) so the test runs without a GPU; on the GPU box bench.py --shard runs the
+(reference getada chain) so the test runs without a GPU; on GPUs bench.py --shard runs the
 same logic with the CUDA kernels and NCCL."""
 import os
 import sys
@@ -11,12 +11,12 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from helpers import ROOT, ref
+from helpers import ROOT, needs_reference
 from sedumi_b200.host import cones, problems, setup, shard
 
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
-needs_ref = pytest.mark.skipif(not ref.has("getada3"), reason="oracle/_ref not built")
+needs_ref = needs_reference("test_shard_cpu", "getada3")
 
 
 def test_partition_is_balanced_and_complete():
@@ -34,6 +34,14 @@ def _worker(rank, world, port, out, compact):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     import refpath
+    import replay
+    caller = os.environ["PYTEST_CURRENT_TEST"].rsplit(" (", 1)[0] + f"/rank{rank}"     # one record per rank
+    with replay.context(caller):
+        _assemble(rank, world, out, compact, refpath)
+    replay.finish(caller)
+
+
+def _assemble(rank, world, out, compact, refpath):
     raw = problems.synth_blockdiag_sdp(nblk=6, n=8, m=40, nlink=5, density=0.15, seed=3)
     At, b, c, K = cones.pretransfo(*raw)[:4]
     S = setup.build_setup(At, b, c, K, perm=np.arange(At.shape[1]))

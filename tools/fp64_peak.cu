@@ -1,5 +1,5 @@
 // Microbenchmark: issue-bound FP64 throughput of DMMA.8x8x4 (mma.sync.m8n8k4.f64) vs plain DFMA on this GPU.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_peak tools/fp64_peak.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_peak tools/fp64_peak.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void dmma_loop(double *out, int iters) {

@@ -1,4 +1,4 @@
-"""Per-phase cycle counts of the fused getada3 kernel on the headline workload (diagnostic; run on the GPU box)."""
+"""Per-phase cycle counts of the fused getada3 kernel on the headline workload (diagnostic; needs a GPU)."""
 import ctypes as C
 import json
 import os
